@@ -1,5 +1,5 @@
 // ik_evolution_2_b200.cpp — the ONE translation unit a bio_ik maintainer adds to the reference tree (next to
-// src/ik_evolution_2.cpp, linked with -lbioik_b200) to run the bio2 family on a B200 behind the reference's own solver seam.
+// src/ik_evolution_2.cpp, linked with -lbioik_b200) to run the bio2 family on an H100 behind the reference's own solver seam.
 //
 // It registers three IKBase subclasses with IKFactory, exactly like src/ik_evolution_2.cpp:652-654 registers the CPU ones:
 //     mode: bio2_b200 | bio2_memetic_b200 | bio2_memetic_l_b200        (ROS parameter read at src/kinematics_plugin.cpp:252-253)

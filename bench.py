@@ -45,6 +45,7 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--cpu-seconds", type=float, default=12.0)
     ap.add_argument("--no-other-configs", action="store_true", help="skip the cfg3/cfg4/cfg5 table of the default cfg2 run")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed pass returned as DIR/<name>.npy (float64)")
     return ap.parse_args()
 
 
@@ -121,7 +122,7 @@ def usable_cpus():
 
 def cpu_solver():
     """(object with .solve(...), kind): the reference's own code built with its Release flags when oracle/_ref/ holds
-    it (built here from /root/reference by __graft_entry__.build(); the prebuilt .so travels to the GPU box), else the
+    it (built by __graft_entry__.build() where the reference's sources are present), else the
     oracle port built with the same flags."""
     import oracle_lib
     if os.path.exists(oracle_lib.ref_lib_path("fast")) and not os.environ.get("BIOIK_BENCH_CPU_PORT"):
@@ -194,21 +195,42 @@ def run_reference(args):
     print(json.dumps(line), flush=True)
 
 
-# algorithmic FP64 flops of one individual-evaluation (SURVEY.md §8(d), FMA = 2) and, where an ncu capture exists, the flops the
-# generation kernel's opcode mix really executes per child (profiles/r01_k_evolve_fast_v7.txt: K1's r * rate * span is tabulated)
+# algorithmic FP64 flops of one individual-evaluation (SURVEY.md §8(d), FMA = 2)
 FLOPS_PER_UNIT = {"cfg1": 252.0, "cfg2": 252.0, "cfg3": 540.0, "cfg4": 1300.0, "cfg5": 924.0}
-EXECUTED_FLOPS_PER_UNIT = {"cfg1": 183.0, "cfg2": 183.0}
 
 
-def fp64_peak(clocks):
-    """(TFLOP/s, source): the FP64-pipe peak measured by profiles/fp64_peak.cu on this pool's B200 (independent DFMA chains, all
+def fp64_peak(clocks, sm_count):
+    """(TFLOP/s, source): the FP64-pipe peak measured by profiles/fp64_peak.cu on an H100 (independent DFMA chains, all
     SMs, CUDA events), else the nominal pipe width at the sampled clock."""
     try:
         d = json.load(open(os.path.join(ROOT, "profiles", "fp64_peak.json")))
         return float(d["fp64_tflops"]), f"profiles/fp64_peak.json (measured with profiles/fp64_peak.cu: independent DFMA chains on every SM at {d['sm_mhz_during_peak']:.0f} MHz; nominal {d['nominal_tflops_at_that_clock']:.1f})"
     except Exception:
-        mhz = (clocks or {}).get("sm_mhz") or 1965.0
-        return 148 * 64 * 2 * mhz * 1e6 / 1e12, "fallback: nominal 148 SMs x 64 FP64 FMA lanes x 2 x sampled SM clock (profiles/fp64_peak.json absent)"
+        mhz = (clocks or {}).get("sm_mhz") or 1980.0
+        return sm_count * 64 * 2 * mhz * 1e6 / 1e12, f"fallback: nominal {sm_count} SMs x 64 FP64 FMA lanes x 2 x sampled SM clock (profiles/fp64_peak.json absent)"
+
+
+DUMP_LIMIT_BYTES = 64 * 1024 * 1024
+
+
+def dump_outputs(path, sharded):
+    """The arrays the timed path hands back, as float64 DIR/<name>.npy: this rank's solutions, fitness, success flags and step
+    counts and, on several GPUs, the gathered [world * B][n_vars + 3] result slab.  Above 64 MB in all (DIR/rows.npy included),
+    a fixed, seeded sample of query indices q within the shard is kept: rows q of the per-rank arrays and rows k * B + q of the
+    gathered slab for every rank k; DIR/rows.npy lists the q."""
+    os.makedirs(path, exist_ok=True)
+    arrays = {"solutions": sharded.sol, "fitness": sharded.fit, "success": sharded.succ, "steps": sharded.steps}
+    if sharded.world > 1:
+        arrays["gathered"] = sharded.gathered
+    arrays = {k: v.detach().to(device="cpu", dtype=sharded.torch.float64).numpy() for k, v in arrays.items()}
+    B, world = sharded.B, sharded.world
+    if sum(a.nbytes for a in arrays.values()) > DUMP_LIMIT_BYTES:
+        per_query = sum(a.nbytes for a in arrays.values()) // B + 8  # every array's rows of one query + its entry in rows.npy
+        q = np.sort(np.random.default_rng(0).permutation(B)[:max(1, (DUMP_LIMIT_BYTES - 128 * (len(arrays) + 1)) // per_query)])  # 128: an .npy header
+        np.save(os.path.join(path, "rows.npy"), q.astype(np.float64))
+        arrays = {k: a[(np.arange(world)[:, None] * B + q[None, :]).reshape(-1)] if k == "gathered" else a[q] for k, a in arrays.items()}
+    for name, a in arrays.items():
+        np.save(os.path.join(path, f"{name}.npy"), np.ascontiguousarray(a))
 
 
 def measure(args, config, B, steps, warmup, env, cpu_seconds, full):
@@ -264,6 +286,8 @@ def measure(args, config, B, steps, warmup, env, cpu_seconds, full):
     barrier()
     t_wall = time.perf_counter() - t_wall0
     clocks = sampler.stop() if sampler else None
+    if full and args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, sharded)
     total_ms = sum(a.elapsed_time(b) for a, b in evs)
     launches = solver.launch_count() - launches0
     ev_ms, ev_n, ser_ms, ser_n = solver.kernel_time(reset=True)
@@ -315,10 +339,10 @@ def measure(args, config, B, steps, warmup, env, cpu_seconds, full):
 
     # Roofline of the dominant kernel.  The population never leaves the chip (genes, gradients, fitness live in registers, the
     # mutation table in L2), so the FP64 pipe binds, not HBM: achieved = algorithmic flops of the generation work / the kernel's
-    # CUDA-event time, peak = the measured DFMA peak.  The HBM view is kept beside it: real DRAM traffic of the kernel (ncu) / its time.
+    # CUDA-event time, peak = the measured DFMA peak.  The HBM peak is kept beside it for reference.
     units = B * 2 * 8 * (args.population - 2) * S * steps       # individual-evaluations inside the timed region (per GPU)
     flops_unit = FLOPS_PER_UNIT.get(config, 252.0)
-    peak_tf, peak_src = fp64_peak(clocks)
+    peak_tf, peak_src = fp64_peak(clocks, torch.cuda.get_device_properties(dev).multi_processor_count)
     roofline = None
     if ev_n:
         ach_tf = units * flops_unit / (ev_ms * 1e-3) / 1e12
@@ -329,29 +353,14 @@ def measure(args, config, B, steps, warmup, env, cpu_seconds, full):
                     "note": "unit = one individual-evaluation (reproduce + approximate phenotype + goal fitness), SURVEY.md §8(d); "
                             + ("the kernel also carries the memetic line search, exact FK, Jacobian and species block of every step, which the algorithmic count does not credit"
                                if persistent else "one launch per step(); the per-task serial work runs in the other kernels")}
-        if config in EXECUTED_FLOPS_PER_UNIT:
-            ex = units * EXECUTED_FLOPS_PER_UNIT[config] / (ev_ms * 1e-3) / 1e12
-            roofline["executed"] = {"flops_per_unit": EXECUTED_FLOPS_PER_UNIT[config], "achieved": ex, "frac": ex / peak_tf,
-                                    "note": "flops of the instructions really issued per child (opcode mix of the ncu capture): K1's r * rate * span is tabulated once per problem"}
         peaks = {}
         try:
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-        hbm = {"peak": hbm_peak, "unit": "GB/s", "peak_source": "MEASURED_PEAKS.json hbm_gbs (measured)" if peaks else "fallback 6650 GB/s", "achieved": None, "frac": None,
-               "algorithmic_bytes_per_unit": 24 * n + 8, "note": "not the bound: the state is L2/shared-memory resident by design; achieved = measured DRAM bytes of the kernel / its time"}
-        tp = os.path.join(ROOT, "profiles", "evolve_traffic.json")
-        if os.path.exists(tp) and config == "cfg2" and args.population == 128 and B == 10000:  # the shape the committed ncu capture was taken on
-            try:
-                tr = json.load(open(tp))
-                if tr.get("kernel", "").split("<")[0] == kernel_name.split("<")[0]:
-                    roofline["traffic"] = tr.get("dram_bytes_per_launch")
-                    hbm["achieved"] = roofline["traffic"] / (ev_ms / ev_n * 1e-3) / 1e9
-                    hbm["frac"] = hbm["achieved"] / hbm_peak
-                    hbm["traffic_source"] = tr.get("source")
-            except Exception:
-                pass
+        hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+        hbm = {"peak": hbm_peak, "unit": "GB/s", "peak_source": "MEASURED_PEAKS.json hbm_gbs (measured)" if peaks else "fallback: 3350 GB/s, H100 SXM data sheet", "achieved": None, "frac": None,
+               "algorithmic_bytes_per_unit": 24 * n + 8, "note": "not the bound: the state is L2/shared-memory resident by design; achieved is not measured (no DRAM counters in this run)"}
         roofline["hbm"] = hbm
     res["roofline"] = roofline
 
@@ -392,7 +401,7 @@ def main():
     stream = torch.cuda.Stream(device=dev)  # the solve, the L2 flush, the events and NCCL all run on this stream
     torch.cuda.set_stream(stream)
     env = dict(torch=torch, dist=dist, world=world, rank=rank, local_rank=local_rank, dev=dev, stream=stream,
-               flush=torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev))  # > 126 MB L2
+               flush=torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev))  # > the 50 MB L2 of an H100
     m = measure(args, args.config, args.batch, args.steps, args.warmup, env, 0.0 if args.no_cpu_baseline else args.cpu_seconds, True)
 
     # BASELINE.json's other configurations on the same box (N = 1 only): GPU value, e2e, the reference's CPU arm and the bound fraction
@@ -401,7 +410,7 @@ def main():
         others = {}
         for name, b in (("cfg3", 4096), ("cfg4", 2048), ("cfg5", 8192)):
             try:
-                o = measure(args, name, b, 3, 3, env, 0.0 if args.no_cpu_baseline else min(args.cpu_seconds, 6.0), False)
+                o = measure(args, name, b, args.steps, args.warmup, env, 0.0 if args.no_cpu_baseline else min(args.cpu_seconds, 6.0), False)
                 c, r = o.get("cpu_baseline"), o.get("roofline")
                 others[name] = {"workload": o["workload"], "batch": b, "value": o["value"], "ms_per_step": o["ms_per_step"], "e2e": o["e2e_value"],
                                 "cpu": c["value"] if c else None, "cpu_cores": c["cores"] if c else None, "cpu_kind": c["kind"] if c else None,

@@ -108,7 +108,7 @@ def load_library(path=None):
     p = path or LIB_PATH
     if not os.path.exists(p):
         raise RuntimeError(
-            f"{p} not found: build the sm_100a extension first (python -c 'import __graft_entry__ as g; g.build()'). "
+            f"{p} not found: build the sm_90a extension first (python -c 'import __graft_entry__ as g; g.build()'). "
             "bio_ik_b200 has no CPU fallback.")
     lib = C.CDLL(p)
     ctx_p = C.c_void_p

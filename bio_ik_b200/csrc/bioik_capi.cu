@@ -60,7 +60,7 @@ struct bioik_ctx
     HostRobot robot;
     cudaStream_t stream = nullptr;
     int serial_plan_force = -1;
-    int lpt_want = 16; // BIOIK_EVOLVE_LPT: lanes per task of the single-pose generation kernel (8, 16 or 32; measured 7.15 / 6.98 / 7.22 ms per cfg2 pass)
+    int lpt_want = 16; // BIOIK_EVOLVE_LPT: lanes per task of the single-pose generation kernel (8, 16 or 32; 16 was the fastest on cfg2)
     int ch_cap = 8; // BIOIK_EVOLVE_CH: cap of the register block of k_evolve_fast (experiments)
     std::string error;
     int64_t launches = 0;
@@ -80,7 +80,7 @@ struct bioik_ctx
     double* d_mtab = nullptr; // [calls][n][C] mutation table of the fast generation kernel
     SerialPlan splan;           // launch plan of the fused serial kernel (set_problem)
     SerialKernel serial = nullptr;
-    int sm_count = 148;
+    int sm_count = 132; // H100 SXM; replaced by the device's own count when the context is created
     bool force_generic = false; // BIOIK_FORCE_GENERIC=1: always use the generic generation kernel (tests)
     bool generic_now = false;   // the solve in flight runs the generic kernels (forced, or a problem shape the fused kernels do not take)
 

@@ -1,4 +1,4 @@
-// bioik_dev.cuh — per-thread device functions of the B200 bio2/bio2_memetic path.
+// bioik_dev.cuh — per-thread device functions of the H100 bio2/bio2_memetic path.
 //
 // Arithmetic contract (DESIGN.md §3): IEEE binary64, no implicit FMA contraction
 // (nvcc -fmad=false), explicit __fma_rn only where the reference's AVX+FMA

@@ -247,7 +247,7 @@ BIOIK_HD void joint_goal_accumulate(int type, int var_index, int i, double x, do
 // min over the LPT lanes of a task.  With 16 lanes per task the two groups of a warp run the two species of ONE query: they enter,
 // loop and leave together, so the reduction is issued warp-wide with a constant full mask - one REDUX per group, back to back.
 // (A group mask known only at run time makes the compiler wrap every warp primitive in mask-matching code and run the groups one
-// after the other: 12 % of the single-pose kernel's time before this form.)
+// after the other.)
 template <int LPT> __device__ __forceinline__ uint32_t group_reduce_min(uint32_t v, unsigned gmask, int lane0)
 {
     if(LPT == 32) return __reduce_min_sync(0xffffffffu, v);
@@ -391,7 +391,7 @@ template <bool JOINT> __device__ __forceinline__ double fast_eval_one_tips(const
 // TM (tip-major form, T must be 1): any number of tips P.T, one tip's frame accumulators at a time over that tip's gene list
 // LPT (lanes per task): 32 = one warp per task; 16 / 8 = two / four tasks per warp, each lane then owns 8 / 16 children.  The
 // per-child work is lane-efficient either way, but the per-generation overhead (tables, the two argmin reductions, winner
-// re-derivation: ~37 % of the instructions at LPT 32) is issued once per WARP, i.e. shared by the tasks of the warp.
+// re-derivation: a large share of the instructions at LPT 32) is issued once per WARP, i.e. shared by the tasks of the warp.
 // The body of the generation kernel for ONE task = (query, species slot): `generations` x {reproduce, phenotype, fitness, selection}
 // of step `step`, run by the LPT lanes `gmask` of a warp (lane = index inside that group, lane0 = its first warp lane) on the
 // shared-memory block W (FastSmem::total() doubles).  Called by k_evolve_fast (one launch per step) and by the persistent
@@ -1130,8 +1130,8 @@ __device__ __forceinline__ void evolve_fast_task(const DProblem& P, const DState
 }
 
 // Launch bounds = the register budget.  The 16-lane single-pose kernels run best at THREE warps per scheduler with 168 registers
-// (no hot-loop spills: 250 us per cfg2 launch; 16 warps per SM at 128 registers with 136 B of spills: 285 us; 14 / 13 / 11 / 10 / 8 warps:
-// 273 / 260 / 293 / 283 / 283 us - profiles/r02_experiments.md §4) in blocks of two warps (finer block granularity in the last wave);
+// (no hot-loop spills; 16 warps per SM at 128 registers spill in the hot loop, and every other warp count from 8 to 14 was slower)
+// in blocks of two warps (finer block granularity in the last wave);
 // the other forms keep four warps per block and the occupancy they were tuned at.
 #ifndef BIOIK_EVOLVE_WPB16
 #define BIOIK_EVOLVE_WPB16 2 // warps per block of the 16-lane kernels
@@ -1194,7 +1194,7 @@ inline EvolveFastKernel select_evolve_fast(const DProblem& P, int C, int ch_cap 
     const bool single_pose = (P.G == 1 && P.goals[0].type == G_POSE && !P.goals[0].secondary && T == 1);
     int cpl = mtab_row(C) / 32; // 1, 2, 4 or 8
     if(cpl > ch_cap) cpl = ch_cap; // experiment knob: smaller register blocks (more chunks, fewer registers)
-    if(J && cpl > 2) cpl = 2;      // joint-space accumulators on top of the frame accumulators: blocks of 4 spill (cfg4: 29.5 vs 21.8 ms per pass)
+    if(J && cpl > 2) cpl = 2;      // joint-space accumulators on top of the frame accumulators: blocks of 4 spill (cfg4 is faster with 2)
 #define BIOIK_PICK(TT, CC) (J ? BIOIK_NAMED_AS(EvolveFastKernel, k_evolve_fast<TT, CC, 0, true>) : BIOIK_NAMED_AS(EvolveFastKernel, k_evolve_fast<TT, CC, 0, false>))
     if(single_pose && (P.n == 7 || P.n == 6) && ch_cap >= 8)
     {
@@ -1213,8 +1213,8 @@ inline EvolveFastKernel select_evolve_fast(const DProblem& P, int C, int ch_cap 
     }
     if(single_pose) return cpl >= 3 ? BIOIK_NAMED_AS(EvolveFastKernel, k_evolve_fast<1, 4, 1, false>) : (cpl == 2 ? BIOIK_NAMED_AS(EvolveFastKernel, k_evolve_fast<1, 2, 1, false>) : BIOIK_NAMED_AS(EvolveFastKernel, k_evolve_fast<1, 1, 1, false>));
     if(T == 1) return cpl >= 3 ? BIOIK_PICK(1, 4) : (cpl == 2 ? BIOIK_PICK(1, 2) : BIOIK_PICK(1, 1));
-    if(!fast_tip_major(P)) return cpl >= 2 ? BIOIK_PICK(2, 2) : BIOIK_PICK(2, 1); // two tips still fit the gene-major register block (cfg3: 9.9 vs 10.1 ms per pass)
-    // three or more tips: the tip-major form (one tip's accumulators at a time, so the register block does not depend on T; cfg5: 54.7 vs 57.6 ms)
+    if(!fast_tip_major(P)) return cpl >= 2 ? BIOIK_PICK(2, 2) : BIOIK_PICK(2, 1); // two tips still fit the gene-major register block (cfg3 is slightly faster that way)
+    // three or more tips: the tip-major form (one tip's accumulators at a time, so the register block does not depend on T; faster on cfg5)
 #define BIOIK_PICK_TM(CC) (J ? BIOIK_NAMED_AS(EvolveFastKernel, k_evolve_fast<1, CC, 0, true, 0, true>) : BIOIK_NAMED_AS(EvolveFastKernel, k_evolve_fast<1, CC, 0, false, 0, true>))
     return cpl >= 3 ? BIOIK_PICK_TM(4) : (cpl == 2 ? BIOIK_PICK_TM(2) : BIOIK_PICK_TM(1));
 #undef BIOIK_PICK_TM

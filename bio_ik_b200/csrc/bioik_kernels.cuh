@@ -1,4 +1,4 @@
-// bioik_kernels.cuh — sm_100a kernels of the batched bio2 / bio2_memetic solver.
+// bioik_kernels.cuh — sm_90a kernels of the batched bio2 / bio2_memetic solver.
 //
 // Work decomposition (DESIGN.md §4): a QUERY is one independent IK problem; a TASK is
 // (query, species slot).  The two species of a query never interact inside a step()

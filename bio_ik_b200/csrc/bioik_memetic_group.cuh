@@ -10,7 +10,7 @@
 //   * the element-wise gene / gradient updates on n lanes,
 // while every VALUE is produced by the same operations in the same order as in the thread-per-task kernel
 // (k_serial, PH_MEMETIC) — the two are interchangeable bit for bit (tests/test_hostsim_parity.py).
-// The thread-per-task version left the SMs with one warp or less each (B = 10 000 queries -> 625 warps on 148 SMs)
+// The thread-per-task version left the SMs with one warp or less each (B = 10 000 queries -> 625 warps on 132 SMs)
 // and paid the full latency of every FP64 operation; here the same batch is 5 000 warps at W = 8.
 #pragma once
 
@@ -110,9 +110,9 @@ inline int memetic_group_width(int n) { return n <= 8 ? 8 : (n <= 16 ? 16 : 32);
 // species one after the other and carries those frames in `carry` (HBM between steps; identity frames at the start, which
 // is what the harness of the reference build pre-fills - a fresh reference solver reads uninitialised memory there).
 // blocks per SM the register allocation aims for: the kernel is a chain of short dependent phases (latency-bound), so more
-// resident warps beat a larger register file per thread (80 registers, no spills; measured: profiles/r02_experiments.md)
+// resident warps beat a larger register file per thread (80 registers, no spills)
 // (the 16-lane form - two tasks per warp, problems of 9 ... 16 variables - is the exception: four blocks with 128 registers run cfg3's
-// memetic phase in 4.5 ms per pass against 4.75 ms at six; the 32-lane form loses 10 % that way)
+// memetic phase faster than six; the 32-lane form loses that way)
 #ifndef BIOIK_MG_MINBLOCKS
 #define BIOIK_MG_MINBLOCKS 6
 #endif

@@ -1,7 +1,7 @@
 // bioik_persist.cuh — the persistent solve kernel: ONE launch runs steps [s0, s1) of every run of a batch.
 //
 // The stepped path launches k_evolve_fast + k_serial once per step().  That costs the tail of every generation launch
-// (2500 blocks on 592 resident slots = 4.22 waves -> 5 rounds), leaves the chip ~85 % idle while the latency-bound serial
+// (a fractional number of waves of blocks), leaves most of the chip idle while the latency-bound serial
 // kernel runs (one warp per scheduler), and round-trips through ~50 launches per solve.  Here the same two bodies
 // (evolve_fast_task, serial_tasks: identical arithmetic, identical results) are work ITEMS that resident warps take from
 // two queues in device memory:

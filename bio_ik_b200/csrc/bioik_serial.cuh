@@ -40,7 +40,7 @@ __host__ __device__ inline int serial_fixed_doubles(const DProblem& P) { return 
 // The kernel is latency-bound (one dependent chain per thread), so what matters is that ALL tasks are
 // resident at once (a second wave doubles the time): blocks of one warp pack best; pick the most
 // on-chip variant whose resident threads per SM cover ceil(tasks / SMs).
-inline SerialPlan make_serial_plan(const DProblem& P, int tasks = 0, int sm_count = 148, size_t smem_per_sm = 227 * 1024)
+inline SerialPlan make_serial_plan(const DProblem& P, int tasks = 0, int sm_count = 132, size_t smem_per_sm = 227 * 1024)
 {
     const int fixed = serial_fixed_doubles(P), dl = 7 * P.T * P.n, fr = 7 * P.L;
     const int need = tasks > 0 ? (tasks + sm_count - 1) / sm_count : 64; // threads per SM for a single wave

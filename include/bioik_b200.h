@@ -1,5 +1,5 @@
 /*
- * bioik_b200.h — C ABI of libbioik_b200.so: the B200-native bio2 / bio2_memetic
+ * bioik_b200.h — C ABI of libbioik_b200.so: the H100-native bio2 / bio2_memetic
  * population loop of TAMS-Group/bio_ik, evaluated for whole batches of
  * independent IK queries on one GPU.
  *
@@ -10,7 +10,7 @@
  * bioik_last_error() returns a human-readable message for the last failure.
  *
  * There is NO CPU fallback behind this ABI: every compute entry point launches
- * sm_100a kernels and fails with BIOIK_E_CUDA if no usable device is present.
+ * sm_90a kernels and fails with BIOIK_E_CUDA if no usable device is present.
  */
 #ifndef BIOIK_B200_H
 #define BIOIK_B200_H

@@ -2,7 +2,7 @@
 // (TEST INFRASTRUCTURE, NOT PRODUCT CODE).
 //
 // One translation unit = the reference's src/ik_evolution_2.cpp + src/problem.cpp + src/ik_parallel.h where they lie under
-// /root/reference (through ref_harness.cpp and the stand-in third-party headers of oracle/shims/, nothing copied) + the
+// the reference checkout (through ref_harness.cpp and the stand-in third-party headers of oracle/shims/, nothing copied) + the
 // adapter exactly as a bio_ik maintainer would add it.  It is linked against libbioik_b200.so and exports the entry points
 // the `-m gpu` tests of tests/test_adapter.py call, so that
 //   * IKFactory::create("bio2_memetic_b200", params) -> initialize(problem) -> step() x k -> getSolution() runs through the

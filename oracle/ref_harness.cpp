@@ -1,6 +1,6 @@
 // ref_harness.cpp — builds the REFERENCE's own bio2 solver (TEST INFRASTRUCTURE, NOT PRODUCT CODE).
 //
-// This translation unit #includes the reference's sources where they lie under /root/reference
+// This translation unit #includes the reference's sources where they lie in the reference checkout (REFERENCE= in oracle/Makefile)
 // (src/ik_evolution_2.cpp, src/problem.cpp and everything they include) — nothing is copied into this
 // repository — against the stand-in third-party headers of oracle/shims/.  It exposes the same batch
 // entry point as the oracle so that

@@ -8,7 +8,7 @@
 // DFMA/DADD/DMUL/DSETP mix in the proportions of the generation kernel.
 //
 // Build + run (done by __graft_entry__.build() / profiles/measure_fp64_peak.sh on the GPU box):
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o profiles/_bin/fp64_peak profiles/fp64_peak.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o profiles/_bin/fp64_peak profiles/fp64_peak.cu
 //   profiles/_bin/fp64_peak > profiles/fp64_peak.json
 #include <cuda_runtime.h>
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Turns an ncu capture (gpurun_out/*.ncu-rep, brought back from the B200 box) into the small text summary that
+"""Turns an ncu capture (*.ncu-rep) into the small text summary that
 is committed under profiles/: launch configuration, time, pipe utilisation, DRAM traffic, stall reasons and the
 executed-instruction mix by opcode and by loop level.  Usage: python profiles/summarize.py <rep | stem of exported csv pages> <units> > out.txt
 `units` = how many work units (warp-generations for k_evolve_fast, warps for k_serial) the capture covers."""

@@ -1,6 +1,6 @@
-"""Generates the committed golden vectors under tests/golden/ from the IEEE-strict CPU oracle
-(oracle/liboracle_strict.so) in THIS container.  The reference itself cannot be built here
-(SURVEY.md §8(c)), so the vectors pin the oracle restatement, not the upstream binary.
+"""Generates the committed golden vectors under tests/golden/*_pop*.npz from the IEEE-strict CPU oracle
+(oracle/liboracle_strict.so): they pin the oracle restatement.  The stored answers of the reference's own code,
+reference_calls.npz, are recorded differently (tests/golden/README.md).
 Run:  python tests/golden/make_golden.py
 """
 import os

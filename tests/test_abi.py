@@ -33,11 +33,11 @@ def test_abi_version_and_struct_sizes(lib):
     assert C.sizeof(_abi.BioikProblem) == 3 * 16 + 3 * 8
 
 
-def test_sm100a_code_and_no_oracle_linkage(lib):
-    """The shipped library carries sm_100a SASS and does not link or reference the oracle."""
+def test_sm90a_code_and_no_oracle_linkage(lib):
+    """The shipped library carries sm_90a SASS and does not link or reference the oracle."""
     import subprocess
     out = subprocess.run(["cuobjdump", "--list-elf", _abi.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
     ldd = subprocess.run(["ldd", _abi.LIB_PATH], capture_output=True, text=True).stdout
     assert "oracle" not in ldd and "hostsim" not in ldd
     syms = subprocess.run(["nm", "-D", _abi.LIB_PATH], capture_output=True, text=True).stdout

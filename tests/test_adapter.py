@@ -1,6 +1,6 @@
 """SURVEY.md §8(b): the drop-in boundary, compiled.  adapter/ik_evolution_2_b200.cpp (the translation unit a bio_ik maintainer adds)
 is built INSIDE the reference's own solver framework - IKBase, IKFactory, Problem, the goal classes, IKParallel where they lie under
-/root/reference, third-party headers from oracle/shims (oracle/adapter_harness.cpp -> oracle/_ref/libbioik_adapter.so, prebuilt here,
+the reference checkout, third-party headers from oracle/shims (oracle/adapter_harness.cpp -> oracle/_ref/libbioik_adapter.so, prebuilt here,
 travels to the GPU box) - and driven through the reference's types:
     IKFactory::create("bio2_memetic_b200") -> initialize(problem) -> step() x k -> getSolution()      (src/ik_base.h:138-154)
     IKParallel(params).solve()                                                                     (src/ik_parallel.h:148-269)
@@ -21,12 +21,12 @@ ADAPTER_LIB = os.path.join(oracle_lib.REF_DIR, "libbioik_adapter.so")
 
 
 def load_adapter():
-    if os.path.exists(os.path.join(oracle_lib.REFERENCE_ROOT, "src", "ik_parallel.h")):
+    if oracle_lib.REFERENCE_ROOT and os.path.exists(os.path.join(oracle_lib.REFERENCE_ROOT, "src", "ik_parallel.h")):
         import __graft_entry__ as ge
         ge.build_cuda()
         subprocess.run(["make", "-C", oracle_lib.ORACLE_DIR, "-s", "adapter"], check=True)
     if not os.path.exists(ADAPTER_LIB):
-        pytest.skip("oracle/_ref/libbioik_adapter.so is not built (needs /root/reference at build time)")
+        pytest.skip("oracle/_ref/libbioik_adapter.so is not built (needs BIOIK_REFERENCE_SRC at build time)")
     lib = C.CDLL(ADAPTER_LIB)
     dp, ip = _abi.c_double_p, _abi.c_int32_p
     RP, PP = C.POINTER(_abi.BioikRobot), C.POINTER(_abi.BioikProblem)

@@ -2,13 +2,14 @@
 
 oracle/_ref/libbioik_ref_strict.so is the reference's src/ik_evolution_2.cpp + src/problem.cpp (with every bio_ik
 header they include: forward_kinematics.h, ik_base.h, utils.h, goal_types.h ...) compiled where they lie under
-/root/reference through oracle/ref_harness.cpp, against the stand-in third-party headers of oracle/shims/.
+the reference's source tree through oracle/ref_harness.cpp, against the stand-in third-party headers of oracle/shims/.
 Every comparison below is BIT-EXACT.  The oracle runs with one switch flipped: libm sin/cos (what the reference
 calls, forward_kinematics.h:95-109) instead of the arithmetic contract's det_sincos, which is the single
 documented numeric deviation of the product path (DESIGN.md §3, <= 2 ulp, tested in test_oracle.py).
 
-The library is built by `make -C oracle ref` (done by __graft_entry__.build()) wherever /root/reference exists;
-where neither the sources nor a prebuilt oracle/_ref/ are present these tests skip.
+The reference's sources are not part of this repository: its answers are stored in tests/golden/reference_calls.npz
+(oracle_lib.StoredReference), recorded from that library with BIOIK_REFERENCE_RECORD, and every test here compares
+against them.
 """
 import numpy as np
 import pytest
@@ -25,10 +26,7 @@ MODES = {"bio2": (0, 16), "bio2_memetic": ("q", 8), "bio2_memetic_l": ("l", 8)}
 
 @pytest.fixture(scope="module")
 def ref():
-    try:
-        return oracle_lib.Reference("strict")
-    except (FileNotFoundError, OSError) as e:
-        pytest.skip(f"reference build not available here: {e}")
+    return oracle_lib.reference()
 
 
 @pytest.fixture(scope="module")
